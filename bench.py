@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- LUBM Q1-Q7 queries/sec (geomean) on B200, with roofline and CPU baseline.
+"""bench.py -- LUBM Q1-Q7 queries/sec (geomean) on H100, with roofline and CPU baseline.
 
 Contract (see DESIGN.md, Measurement):
   step     = one pass over the query mix Q1..Q7 (each query executed once)
   N = 1    : LUBM-2560 on one GPU (BASELINE config 3)
-  N > 1    : LUBM-10240 sharded by vid % N over the N GPUs (BASELINE config 4, optimal10240_plan), exchange through
+  N > 1    : LUBM-5120 sharded by vid % N over the N GPUs (optimal10240_plan), exchange through
              the single-pass peer-memory push over NVLink; `replicas` (LUBM-2560 on every GPU) and the single-GPU run of
-             the same LUBM-10240 store are secondary keys of the same line.  --mode replicas restores round 1's default.
+             the same LUBM-5120 store are secondary keys of the same line.  --mode replicas restores round 1's default.
   value    = geomean over Q1..Q7 of 1 / mean latency, blind mode (= the reference's global_silent=1 protocol), store and
              plan resident in HBM: CUDA events on the engine's stream for every query that runs as kernel launches; light
              queries answered by the RESIDENT server kernel have no launch to bracket with events, so their term is the
@@ -249,7 +249,7 @@ def cpu_engine_kind(args):
     if REF.available():
         return "reference"
     if want == "reference":
-        raise RuntimeError("oracle/_ref/libwukong_ref.so is missing: run `make -C oracle ref` where /root/reference exists")
+        raise RuntimeError("oracle/_ref/libwukong_ref.so is missing: build it with `make -C oracle ref REFERENCE=<wukong checkout>`")
     return "port"
 
 
@@ -340,10 +340,10 @@ def peak_hbm():
         pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(pk["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
-NVLINK_PEAK_GBS = 770.0   # B200_PROFILING.md: measured peer copy per direction per GPU on this pool (900 nominal)
+NVLINK_PEAK_GBS = 450.0   # H100 SXM data sheet: NVLink 4, 900 GB/s per GPU both directions together
 
 
 def workload_name(args, world, sharded):
@@ -597,7 +597,7 @@ def run_sharded(args, rank, world, local_rank, dist):
                     "achieved_gbs_per_gpu_per_direction": round(per_gpu, 1), "peak_gbs": NVLINK_PEAK_GBS,
                     "frac": round(per_gpu / NVLINK_PEAK_GBS, 4),
                     "note": "bytes stored into peers' buffers (4*C*rows pushed, SURVEY 8d) / summed ready->push->wait time of the heavy queries' "
-                            "exchanges, barriers included; peak = measured peer copy per direction (B200_PROFILING.md), 900 GB/s nominal"}
+                            "exchanges, barriers included; peak = NVLink 4 per direction (H100 SXM data sheet)"}
     t = torch.tensor([np.mean(dev_us[q]) for q in QUERIES] + [np.mean(wall_us[q]) for q in QUERIES] + [np.mean(e2e_us[q]) for q in QUERIES] +
                      [1.0 if resident.get(q) else 0.0 for q in QUERIES], device="cuda", dtype=torch.float64)
     # samples far off their query's median (a descheduled host thread stalls every rank of a collective query): reported, not removed
@@ -710,11 +710,14 @@ def run_single(args, rank, world, local_rank, dist, cpu_arm=True):
             blind_wall_us[q].append(float(w[0]))
             resident[q] = bool(eng.get_option(capi.WK_INFO_LAST_RESIDENT))
     eng.set_profiling(0)
-    for _ in range(args.steps):
+    last_tables = {}
+    for it in range(args.steps):
         for q in QUERIES:
             pats, nvars, req = plans[q]
-            w, _, _, _ = host.time_query(eng, pats, nvars, req, 1, blind=False, table=out_tbl, flush=True)
+            w, _, r, c = host.time_query(eng, pats, nvars, req, 1, blind=False, table=out_tbl, flush=True)
             e2e_us[q].append(float(w[0]))
+            if args.dump_outputs and it == args.steps - 1:
+                last_tables[q] = out_tbl[: r * c].reshape(r, c).copy()
     barrier()
     t_region = time.time() - t_region0
     clocks = sampler.stop()
@@ -829,7 +832,31 @@ def run_single(args, rank, world, local_rank, dist, cpu_arm=True):
                                                "non_blind": {"q%d" % q: round(res[q]["non_blind_us"], 2) for q in QUERIES}}}
     eng.close()
     gst.close()
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_tables)
     return line if rank == 0 else None
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(path, tables):
+    """Writes the full row counts of the last timed end-to-end step as <path>/rows.npy and the result table of every query
+    that returned rows as <path>/q<N>.npy (float64, exact for u32 ids); a query without rows is fully described by its
+    count, so it has no table file.  The engine returns rows in no fixed order, so each table is sorted lexicographically;
+    a table above its share of DUMP_BYTES is cut to a seeded sample of its sorted rows, the same sample for the same table."""
+    os.makedirs(path, exist_ok=True)
+    cap = DUMP_BYTES // len(QUERIES) // 8
+    for q in QUERIES:
+        t = tables[q]
+        if not t.size:
+            continue
+        t = t[np.lexsort(t.T[::-1])]
+        if t.size > cap:
+            keep = np.random.default_rng(q).choice(t.shape[0], cap // t.shape[1], replace=False)
+            t = t[np.sort(keep)]
+        np.save(os.path.join(path, "q%d.npy" % q), t.astype(np.float64))
+    np.save(os.path.join(path, "rows.npy"), np.array([tables[q].shape[0] for q in QUERIES], dtype=np.float64))
 
 
 def ncu_traffic(args, q, step, kind):
@@ -888,6 +915,9 @@ def main():
     ap.add_argument("--mode", default="auto", choices=["auto", "replicas", "sharded"],
                     help="N>1: sharded (vid %% N, exchange over NVLink; the default) or replicas (whole store per GPU, weak scaling)")
     ap.add_argument("--no-secondary", action="store_true", help="N>1 sharded: skip the single-GPU run of the same store and the replicas run")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the row counts of the last timed step to DIR/rows.npy and every non-empty result table to DIR/q<N>.npy "
+                         "(sorted rows, float64, 64 MB at most)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
@@ -896,8 +926,11 @@ def main():
     if args.mode == "auto":
         args.mode = "sharded" if args.gpus > 1 else "replicas"
     sharded = args.gpus > 1 and args.mode == "sharded"
+    if args.dump_outputs and (sharded or args.impl == "reference"):
+        ap.error("--dump-outputs writes the tables of the single-store GPU run; it is not available sharded or with --impl reference")
     if not args.scale:
-        args.scale = 10240 if sharded else 2560     # BASELINE configs 4 and 3
+        # sharded: LUBM-5120 (a ~30 GB store), so that the single-GPU run of the same store still fits one 80 GB H100
+        args.scale = 5120 if sharded else 2560
     if not args.plan:
         args.plan = "optimal10240_plan" if sharded else "osdi16_plan"
     if world > 1:   # torchrun pins OMP_NUM_THREADS=1; the host-side store build is OpenMP-parallel

@@ -1,5 +1,5 @@
 /*
- * wukong_b200 — C ABI of the B200-native graph-exploration engine.
+ * wukong_b200 — C ABI of the H100-native (sm_90a) graph-exploration engine.
  *
  * This is the drop-in boundary for ONE path of SJTU-IPADS/wukong: per-triple-pattern frontier
  * expansion over the predicate-indexed cluster-hash graph store.  The reference has no plugin

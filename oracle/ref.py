@@ -1,7 +1,8 @@
 """TEST INFRASTRUCTURE ONLY: ctypes access to oracle/_ref/libwukong_ref.so -- the reference's OWN store (StaticGStore) and
-query engine (SPARQLEngine) compiled from /root/reference behind C shims (oracle/ref_store_shim.cpp, ref_engine_shim.cpp,
-third-party stand-ins in oracle/ref_stubs/).  Exists only where `make -C oracle ref` has run (the build container; the
-.so travels to the GPU box with the snapshot).  Used to pin the oracle; never by the product."""
+query engine (SPARQLEngine) compiled from a Wukong source checkout ($WUKONG_REFERENCE) behind C shims
+(oracle/ref_store_shim.cpp, ref_engine_shim.cpp, third-party stand-ins in oracle/ref_stubs/).  Exists only where
+`make -C oracle ref REFERENCE=...` has run.  Used to pin the oracle and to make the fixtures under tests/golden/; never by
+the product."""
 import ctypes as C
 import os
 
@@ -68,11 +69,18 @@ class RefGpuEngine:
         return rc, rows.value, cols.value, tbl
 
 
+def reference_tree():
+    """the Wukong source checkout named by $WUKONG_REFERENCE, or None"""
+    p = os.environ.get("WUKONG_REFERENCE", "")
+    return p if p and os.path.isdir(os.path.join(p, "core")) else None
+
+
 def build():
-    """(re)build oracle/_ref when the reference tree is present; returns availability"""
-    if os.path.isdir("/root/reference/core"):
+    """(re)build oracle/_ref when a reference tree is given ($WUKONG_REFERENCE); returns availability"""
+    ref = reference_tree()
+    if ref:
         import subprocess
-        subprocess.check_call(["make", "-C", HERE, "ref"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+        subprocess.check_call(["make", "-C", HERE, "ref", "REFERENCE=" + ref], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
     return available()
 
 

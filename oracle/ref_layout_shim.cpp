@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY.  Compiles the reference's OWN headers (core/store/vertex.hpp,
-// utils/math.hpp, core/type.hpp -- read in place from /root/reference, never copied) behind a tiny
+// utils/math.hpp, core/type.hpp -- read in place from a Wukong checkout, never copied) behind a tiny
 // C interface, so that the key / pointer bit layout, the hash functions, the bucket-count prime
 // table, the id classes and the triple sort orders of oracle and product can be checked against
 // the reference's compiled code.  This pins the DATA-STRUCTURE layer only: the store build and the
@@ -9,7 +9,7 @@
 #include <stdint.h>
 #include <string.h>
 
-#include "store/vertex.hpp"   // -I /root/reference/core -I /root/reference/utils
+#include "store/vertex.hpp"   // -I $(REFERENCE)/core -I $(REFERENCE)/utils
 
 static_assert(sizeof(ikey_t) == 8 && sizeof(iptr_t) == 8 && sizeof(vertex_t) == 16 && sizeof(edge_t) == 4,
               "reference slot / edge sizes");

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY -- shared prologue of oracle/ref_store_shim.cpp and oracle/ref_engine_shim.cpp.
-// Pulls the reference's OWN sources (read in place from /root/reference, never copied) on top of the std-based stand-ins
+// Pulls the reference's OWN sources (read in place from a Wukong checkout, never copied) on top of the std-based stand-ins
 // for Boost / TBB / ZeroMQ in oracle/ref_stubs/ (see ref_stubs/README.md).  The stand-ins and the standard library are
 // included first, so that the access hack below only opens the reference's own classes.
 #pragma once

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY.  The reference's OWN graph store -- core/store/static_gstore.hpp + gstore.hpp + meta.hpp
-// + vertex.hpp + mem.hpp, read in place from /root/reference, never copied -- compiled against the std-based
+// + vertex.hpp + mem.hpp, read in place from a Wukong checkout, never copied -- compiled against the std-based
 // stand-ins for Boost / TBB / ZeroMQ in oracle/ref_stubs/ (those libraries are not in this image; see
 // ref_stubs/README.md), behind a small C interface: build a store from id triples exactly as the loader hands
 // them to StaticGStore::init (base_loader.hpp:308-378: partition by owner and engine, PSO / POS sort with the

@@ -21,7 +21,7 @@
 // Further, independent checks: the gsck invariants (gchecker.hpp:132-360) restated in wko_store_check, and a brute-force
 // triple-scan joiner (tests/sparql_mini.py) on LUBM and on random graphs.
 //
-// All file:line citations are relative to /root/reference/.
+// All file:line citations are relative to the root of a Wukong checkout.
 // =============================================================================================
 #include <algorithm>
 #include <atomic>

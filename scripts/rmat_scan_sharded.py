@@ -42,8 +42,8 @@ if world > 1:
 try:
     peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
-    peak = 6650.0
-NVLINK = 770.0     # measured peer copy per direction per GPU (B200_PROFILING.md); 900 GB/s nominal
+    peak = 3350.0    # H100 SXM data sheet
+NVLINK = 450.0     # H100 SXM data sheet: NVLink 4, 900 GB/s per GPU both directions together
 P = datagen.RMAT_PRED
 t0 = time.time()
 tr = datagen.rmat(args.scale, args.edges, seed=42, typed=False)

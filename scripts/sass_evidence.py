@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Counts, per kernel of libwukong_b200.so, the SASS instructions that prove which data-movement hardware a kernel uses
-(cuobjdump -sass, sm_100a): UBLKCP (cp.async.bulk, the TMA engine's 1-D copies), SYNCS (mbarrier), LDGSTS (cp.async),
+(cuobjdump -sass, sm_90a): UBLKCP (cp.async.bulk, the TMA engine's 1-D copies), SYNCS (mbarrier), LDGSTS (cp.async),
 ACQBULK (griddepcontrol.wait of programmatic dependent launch), ATOMG...SYS (remote reservations over NVLink), CCTL.IVALL (L1
-invalidation of a gpu / system fence), MATCH.ANY (the warp-level owner grouping of the exchange), STG.E.128 (its 16-byte stores).  Writes the markdown table of profiles/r2_sass_evidence.md to stdout."""
+invalidation of a gpu / system fence), MATCH.ANY (the warp-level owner grouping of the exchange), STG.E.128 (its 16-byte stores).  Writes the markdown table of profiles/sass_evidence.md to stdout."""
 import collections
 import os
 import re
@@ -29,8 +29,8 @@ for line in txt.split("\n"):
     m = PAT.search(line)
     if m:
         counts[cur][m.group(1)] += 1
-print("# SASS evidence of the data-movement instructions in libwukong_b200.so (cuobjdump -sass, sm_100a), round 2\n")
-print("Regenerate: `python scripts/sass_evidence.py > profiles/r2_sass_evidence.md`.  Kernels with none of these instructions are left out;")
+print("# SASS evidence of the data-movement instructions in libwukong_b200.so (cuobjdump -sass, sm_90a)\n")
+print("Regenerate: `python scripts/sass_evidence.py > profiles/sass_evidence.md`.  Kernels with none of these instructions are left out;")
 print("the template instances of one kernel that show the same counts are folded into one row.\n")
 print("| kernel | instruction | count |\n|---|---|---|")
 folded = collections.OrderedDict()

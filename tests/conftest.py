@@ -14,7 +14,7 @@ PLANS = ["osdi16_plan", "optimal2560_plan", "optimal10240_plan"]
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _ensure_built():

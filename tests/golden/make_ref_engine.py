@@ -2,7 +2,7 @@
 `make -C oracle ref`): LUBM-1 (wukong_b200.datagen.lubm(1, seed=1)), Q1-Q7 x 3 plan sets -> row count and sha256 of the
 lexicographically sorted result table, plus the same under DISTINCT OFFSET 1 LIMIT 40 (exact order).
 
-    make -C oracle ref && python tests/golden/make_ref_engine.py
+    make -C oracle ref REFERENCE=<wukong checkout> && python tests/golden/make_ref_engine.py
 """
 import hashlib
 import json

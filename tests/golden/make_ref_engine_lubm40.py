@@ -4,7 +4,7 @@ sets -> row count, column count, sha256 of the lexicographically sorted result t
 digest (oracle.ref.table_digest) that bench.py also uses at LUBM-2560.  The store is the reference's own StaticGStore
 build of the same triples.
 
-    make -C oracle ref && python tests/golden/make_ref_engine_lubm40.py
+    make -C oracle ref REFERENCE=<wukong checkout> && python tests/golden/make_ref_engine_lubm40.py
 """
 import hashlib
 import json

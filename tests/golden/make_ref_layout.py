@@ -1,8 +1,8 @@
 """Generates tests/golden/ref_layout.json from the reference's OWN compiled headers
-(oracle/_ref/libwukong_ref_layout.so, built by `make -C oracle ref` from /root/reference/core/store/vertex.hpp,
-utils/math.hpp and core/type.hpp).  Run in the build container (the reference tree is not on the GPU box):
+(oracle/_ref/libwukong_ref_layout.so, built by `make -C oracle ref` from core/store/vertex.hpp of a Wukong checkout,
+utils/math.hpp and core/type.hpp).  Run where a Wukong checkout is available:
 
-    make -C oracle ref && python tests/golden/make_ref_layout.py
+    make -C oracle ref REFERENCE=<wukong checkout> && python tests/golden/make_ref_layout.py
 """
 import ctypes as C
 import json

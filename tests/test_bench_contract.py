@@ -1,6 +1,6 @@
-"""CPU: the JSON line bench.py prints -- keys and types the driver reads.  The reference arm runs here (tiny scale); the
-GPU arm's line is checked on the committed output of the round's 1-GPU run (profiles/r2_bench_lubm2560.json) and, when
-present, on the committed sharded lines (profiles/r2_bench_sharded_*gpu_lubm10240.json)."""
+"""CPU: the JSON line bench.py prints -- keys and types a consumer reads.  The reference arm runs here (tiny scale); the
+GPU arm's line is checked on the committed output of a 1-GPU run on an H100 (profiles/bench_lubm2560_h100.json) and, when
+present, on committed sharded lines (profiles/r2_bench_sharded_*gpu_lubm10240.json)."""
 import json
 import os
 import subprocess
@@ -38,7 +38,7 @@ def test_reference_arm_prints_one_json_line():
 
 
 def test_committed_gpu_line_has_the_contract_keys():
-    d = json.load(open(os.path.join(ROOT, "profiles", "r2_bench_lubm2560.json")))
+    d = json.load(open(os.path.join(ROOT, "profiles", "bench_lubm2560_h100.json")))
     _check_base(d)
     assert "impl" not in d or d["impl"] != "reference"
     assert d["n_gpus"] == 1 and d["dtype"] == "u32" and d["data"] == "synthetic" and d["gpu_launches"] > 0

@@ -67,10 +67,10 @@ def test_triple_sort_orders():
 
 def test_fixture_matches_live_reference_headers():
     from oracle import ref as REF
-    REF.build()                      # builds oracle/_ref where the reference tree is present
+    REF.build()                      # builds oracle/_ref where $WUKONG_REFERENCE names a Wukong checkout
     lib = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "libwukong_ref_layout.so")
     if not os.path.exists(lib):
-        pytest.skip("oracle/_ref not built (the reference tree only exists in the build container)")
+        pytest.skip("oracle/_ref not built (needs a Wukong checkout in $WUKONG_REFERENCE)")
     L = C.CDLL(lib)
     u64 = C.c_uint64
     for n, k in (("ref_key_raw", 3), ("ref_key_hash", 3), ("ref_ptr_raw", 3), ("ref_hash_u64", 1), ("ref_hash_prime_u64", 1)):

@@ -133,7 +133,7 @@ def _spill_want(tr):
 
 
 # ---- the same sharded execution with all shards on ONE GPU: engines of this process as a peer-memory group
-# (wk_comm_local_group), one host thread per rank.  Runs on the single-GPU box the driver uses for `-m gpu`. ----------
+# (wk_comm_local_group), one host thread per rank.  Runs on a single GPU under `-m gpu`. ----------
 def _local_group(world, univs=2, seed=7, rbuf=128 << 20):
     from wukong_b200 import host
     stores, engs = [], []

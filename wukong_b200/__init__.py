@@ -1,4 +1,4 @@
-"""wukong_b200 — B200-native graph-exploration engine behind Wukong's query/plan surface.
+"""wukong_b200 — H100-native (sm_90a) graph-exploration engine behind Wukong's query/plan surface.
 
 The product is native: CUDA kernels + a C ABI (include/wukong_b200.h) in libwukong_b200.so and a
 C++ host layer (reference-surface mirror, store builder, data generators) in libwukong_host.so.

@@ -1,10 +1,10 @@
 """In-tree native build of the wukong_b200 libraries (explicit nvcc / g++; no JIT cache).
 
-  libwukong_b200.so   CUDA kernels for sm_100a + the C-ABI declared in include/wukong_b200.h
+  libwukong_b200.so   CUDA kernels for sm_90a (H100) + the C-ABI declared in include/wukong_b200.h
   libwukong_host.so   host-side C++ (reference-surface mirror, store builder, data generators),
                       linked against libwukong_b200.so
 
-Both are written next to this file so they travel with the repo snapshot to the GPU box.
+Both are written next to this file, where capi.py and host.py load them from.
 """
 import os
 import shutil
@@ -21,7 +21,7 @@ LIB_HOST = os.path.join(HERE, "libwukong_host.so")
 CUDA_SOURCES = ["kernels/engine.cu", "kernels/store_build.cu", "kernels/table_ops.cu"]
 HOST_SOURCES = ["datagen/lubm_gen.cpp", "datagen/rmat_gen.cpp", "store/host_builder.cpp", "host/host_capi.cpp"]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xcompiler", "-fopenmp", "-shared",
               "-cudart", "static"]
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-fopenmp", "-shared", "-Wall", "-Wno-sign-compare", "-pthread"]
@@ -73,8 +73,7 @@ def build_host(force=False):
     deps = _deps([os.path.join(CSRC, "datagen"), os.path.join(CSRC, "store"), os.path.join(CSRC, "host"), INCLUDE])
     if not force and not _newer(LIB_HOST, deps + [__file__]):
         return LIB_HOST
-    # NOTE: $CXX in this image is a wrapper that links libstdc++ statically (breaks iostreams in a
-    # dlopen()ed library); always use the system g++.
+    # the system g++: a $CXX wrapper that links libstdc++ statically breaks iostreams in a dlopen()ed library
     cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else (shutil.which("g++") or "g++")
     cmd = [cxx] + CXX_FLAGS + ["-I", INCLUDE, "-I", CSRC] + srcs + ["-o", LIB_HOST]
     # the host library calls the GPU engine through the C-ABI only

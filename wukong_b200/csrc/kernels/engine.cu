@@ -1,6 +1,6 @@
-// wukong_b200 GPU engine: kernels + C-ABI (include/wukong_b200.h).  sm_100a only.
+// wukong_b200 GPU engine: kernels + C-ABI (include/wukong_b200.h).  sm_90a (H100) only.
 //
-// Design (B200-first, not a port of the reference's core/gpu):
+// Design (H100-first, not a port of the reference's core/gpu):
 //   * the whole cluster-hash store lives in flat HBM arrays (no segment paging / block maps);
 //   * one fused kernel per pattern step: probe -> multiplicity -> tile scan -> materialise,
 //     persistent grid sized from the SM count, row counts stay on the device between steps
@@ -560,7 +560,7 @@ struct wk_engine {
     int profiling = 0;   // 0 off, 1 query-level CUDA events, 2 also per-step events
     cudaEvent_t q_ev0 = nullptr, q_ev1 = nullptr;
     bool q_timed = false;
-    int num_sms = 148;
+    int num_sms = 132;
     int occ[3] = {1, 1, 1};
     int variant = 1;
     uint64_t launches = 0;
@@ -590,12 +590,12 @@ struct wk_engine {
         bool sharded = false;            // the last instance launched is the sharded server (peer view, verdict flags)
         uint64_t launches = 0, requests = 0;
         uint64_t last_ns = 0;            // in-kernel span of the last request
-        int variant = 0;                 // WK_OPT_RESIDENT_VARIANT (default 0; A/B on B200 in profiles/r2_light_ab.json): 0 = 1024 threads + warp mode, 1 = 256 + warp mode, 2 = 256, block steps only, 3 = 512 + warp mode
+        int variant = 0;                 // WK_OPT_RESIDENT_VARIANT (default 0): 0 = 1024 threads + warp mode, 1 = 256 + warp mode, 2 = 256, block steps only, 3 = 512 + warp mode
     } srv;
     bool last_resident = false;          // the last wk_query_execute was answered by the resident server
-    // WK_OPT_DIRECT_OUT: last step writes projected rows into the caller's pinned buffer.  Off by default: measured on B200
-    // (LUBM-2560), row-sized stores from the expand kernel cross PCIe at 6-12 GB/s (Q2: 1 879 us against 543 us for
-    // projection + one 52 GB/s copy); it only pays for results of a few thousand rows (Q1: -8 us).
+    // WK_OPT_DIRECT_OUT: last step writes projected rows into the caller's pinned buffer.  Off by default: row-sized
+    // stores from the expand kernel cross PCIe far slower than one bulk copy of the projected table; it only pays for
+    // results of a few thousand rows.
     bool direct_out = false;
     const void *dout_host = nullptr;     // last caller buffer examined, and its device address (nullptr: not device-accessible)
     uint32_t *dout_dev = nullptr;
@@ -2277,9 +2277,9 @@ __global__ void flush_read_kernel(const uint4 *p, size_t n, uint32_t *sink) {
     if (acc == 0x12345679u) *sink = acc;   // never true in practice; keeps the loads alive
 }
 
-// Evict the L2 between timed iterations: overwrite a scratch buffer larger than the 126 MB L2, then read
+// Evict the L2 between timed iterations: overwrite a scratch buffer several times the 50 MB L2, then read
 // 256 MB of it back so that the cache is left full of CLEAN foreign lines (a write-only flush leaves
-// 126 MB of dirty lines whose write-back would be charged to the next timed query).
+// an L2 full of dirty lines whose write-back would be charged to the next timed query).
 int wk_engine_flush_l2(wk_engine_t *e) {
     if (!e) return WK_ERR_BAD_ARG;
     CUDA_TRY(cudaSetDevice(e->store->device));

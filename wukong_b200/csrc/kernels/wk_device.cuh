@@ -1,7 +1,7 @@
-// Device-side building blocks of the frontier-expansion engine (sm_100a).
+// Device-side building blocks of the frontier-expansion engine (sm_90a).
 //
 // Semantics follow the reference's probe (store/gstore.hpp:242-248, 341-361, 393-410) and key
-// layout (store/vertex.hpp:47-66, 116-119); the implementation is a B200-first design:
+// layout (store/vertex.hpp:47-66, 116-119); the implementation is an H100-first design:
 //   * a bucket is 8 x 16 B = 128 B = one L2/HBM line: 8 lanes fetch it with one LDG.128 each
 //     (one wavefront per probe), 4 probes per warp instruction, 8 instructions in flight per warp;
 //   * the per-segment modulo is a multiply-shift (no 64-bit division on the device);

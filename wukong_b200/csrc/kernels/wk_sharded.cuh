@@ -259,9 +259,9 @@ __device__ __forceinline__ void push_run(uint32_t *dst, const uint32_t *src, uin
 // earlier kernels are done, and every CTA waits for all peers' word before its first store into a peer's buffer.  Only for
 // ranks on different devices: on a shared device a grid of waiting CTAs could keep a peer's kernel from becoming resident.
 //
-// Pipeline of a CTA (measured on 2 B200s, scripts/exchange_bench.py --variants: with the reservations and the remote stores
-// switched off the first version of this kernel still took 3/4 of its time -- it was bound by its own load -> sync -> rank ->
-// sync -> reserve -> sync -> stage -> sync -> store -> sync chain, 13 us per tile, not by NVLink):
+// Pipeline of a CTA (scripts/exchange_bench.py --variants: with the reservations and the remote stores switched off the
+// first version of this kernel still took most of its time -- it was bound by its own load -> sync -> rank -> sync ->
+// reserve -> sync -> stage -> sync -> store -> sync chain, not by NVLink):
 //   * tiles are fetched with 16-byte cp.async into a double buffer: tile i + 1 is in flight while tile i is grouped;
 //   * three barriers per tile: rows landed | ranks known | staged; every warp derives the run offsets it needs from the
 //     tile's histogram by a shuffle scan, only warp 0 publishes them (and reserves) for the store phase;
